@@ -80,6 +80,7 @@ def load():
         ("b2f_canny_host", [vp, vp, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, vp, ip]),
         ("b2f_canny_batch", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, vp, vp]),
         ("b2f_canny_dev", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, vp, vp, vp]),
+        ("b2f_canny_hysteresis_dev", [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
         ("b2f_canny_stats", [vp, C.POINTER(C.c_ulonglong)]),
         ("b2f_fhog_size", [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, ip, ip]),
         ("b2f_fhog_host", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp]),
@@ -167,7 +168,7 @@ EXPORTS = [
     "b2f_init", "b2f_shutdown", "b2f_last_error", "b2f_version", "b2f_device_count", "b2f_free", "b2f_stream",
     "b2f_launch_count", "b2f_set_chunk_bytes", "b2f_harris_default_params", "b2f_harris_host", "b2f_harris_batch_u8",
     "b2f_harris_response_dev", "b2f_harris_nms_dev", "b2f_harris_corners_dev", "b2f_harris_cert_stats",
-    "b2f_harris_response_eps_dev", "b2f_canny_host", "b2f_canny_batch", "b2f_canny_dev", "b2f_canny_stats",
+    "b2f_harris_response_eps_dev", "b2f_canny_host", "b2f_canny_batch", "b2f_canny_dev", "b2f_canny_hysteresis_dev", "b2f_canny_stats",
     "b2f_fhog_size", "b2f_fhog_host", "b2f_fhog_batch", "b2f_fhog_dev", "b2f_surf_host", "b2f_surf_batch", "b2f_surf_dev",
     "b2f_otsu_host", "b2f_otsu_batch_u8", "b2f_otsu_dev",
     "b2f_harris_host_r64", "b2f_canny_host_r32", "b2f_fhog_host_r32", "b2f_surf_host_r32", "b2f_features_batch_rgb", "b2f_features_batch_grey", "b2f_lsd_front_size", "b2f_lsd_front_host", "b2f_lsd_front_dev",

@@ -66,6 +66,14 @@ def canny_dev(d_frames, n_frames, nx, ny, d_edges, d_nonzero, s=2.0, low_thr=3.0
                                  _lib.ptr(stream) if stream is not None else None))
 
 
+def canny_hysteresis_dev(d_cls, n_frames, nx, ny, d_edges, d_nonzero, stream=None, ctx=None):
+    """The hysteresis stage alone on device-resident class maps (uint8 [n, ny, nx]: 0 = no edge, 2 = strong,
+    any other non-zero = weak) -> edge map (0 / 255) and per-frame edge counts, as canny_dev writes them."""
+    lib = _lib.load()
+    _lib.check(lib.b2f_canny_hysteresis_dev(ctx or _lib.context(), _lib.ptr(d_cls), n_frames, nx, ny, _lib.ptr(d_edges),
+                                            _lib.ptr(d_nonzero), _lib.ptr(stream) if stream is not None else None))
+
+
 def canny_tier2_pixels(ctx=None):
     """Pixels of this context's Canny calls that went to the exact fp64 tier (b2f_canny_stats)."""
     lib = _lib.load()

@@ -848,6 +848,23 @@ hyst_emit_kernel(const unsigned *__restrict__ E, const unsigned char *__restrict
   }
 }
 
+// Class bytes -> the tile-major masks E, S that canny_grad_nms_spec2_kernel writes (b2f_canny_hysteresis_dev only).
+// Same grid as the NMS kernel, one ballot pair per tile row; pixels outside the image give 0 bits.
+__global__ void __launch_bounds__(256)
+hyst_pack_kernel(const unsigned char *__restrict__ cls, unsigned *__restrict__ emask, unsigned *__restrict__ smask, int nx, int ny) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int gx = blockIdx.x * HT + lane;
+  const unsigned char *src = cls + (size_t)blockIdx.z * nx * ny;
+  const size_t t = ((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
+#pragma unroll
+  for (int k = 0; k < HT / 8; k++) {
+    const int ly = warp + 8 * k, gy = blockIdx.y * HT + ly;
+    const unsigned char c = (gx < nx && gy < ny) ? __ldg(src + (size_t)gy * nx + gx) : (unsigned char)0;
+    const unsigned e = __ballot_sync(0xffffffffu, c != 0), s = __ballot_sync(0xffffffffu, c == 2);
+    if (lane == 0) { emask[HT * t + ly] = e; smask[HT * t + ly] = s; }
+  }
+}
+
 // ------------------------------------------------------------------------------------------ host
 // tap list of one axis: orc_canny_taps restated (tools.c:146-163): wrap coordinates, exp(-c^2/s^2),
 // unit sum over the full period, taps below 2^-64 dropped.
@@ -875,31 +892,71 @@ static bool symmetric_taps(const std::vector<int> &c, const std::vector<double> 
   return true;
 }
 
+// Scratch of the hysteresis stage for `tiles` 32x32 tiles, the edge and strong masks included.
+static size_t hyst_scratch_bytes(size_t tiles) {
+  return 2 * align256(tiles * HT * 4) /*edge, strong masks*/ + align256(tiles * HT * HYST_MAX_RUNS) /*runc*/ +
+         align256(tiles * 4) /*ncomp*/ + align256(tiles * HYST_MAX_ROOTS * 4) /*parent*/ + 2 * align256(tiles * HYST_MAX_ROOTS) /*strong, keep*/;
+}
+static size_t hyst_tile_count(int n_frames, int nx, int ny) { return (size_t)ceil_div(nx, HT) * ceil_div(ny, HT) * n_frames; }
+
 size_t canny_scratch_bytes(int n_frames, int nx, int ny) {
-  const size_t n = (size_t)n_frames * nx * ny, tiles = (size_t)ceil_div(nx, HT) * ceil_div(ny, HT) * n_frames;
-  return align256(n * 4) /*blur*/ + 2 * align256(tiles * HT * 4) /*edge, strong masks*/ + align256(tiles * HT * HYST_MAX_RUNS) /*runc*/ +
-         align256(tiles * 4) /*ncomp*/ + align256(tiles * HYST_MAX_ROOTS * 4) /*parent*/ + 2 * align256(tiles * HYST_MAX_ROOTS) /*strong, keep*/ +
+  const size_t n = (size_t)n_frames * nx * ny;
+  return align256(n * 4) /*blur*/ + hyst_scratch_bytes(hyst_tile_count(n_frames, nx, ny)) +
          align256(n * 8) /*blur row sums (generic path rows)*/ + (1 << 16) /*generic path tap lists*/;
 }
 
-int canny_device(b2f_ctx *ctx, const unsigned char *d_frames, int n_frames, int nx, int ny, double s, double low_thr,
-                 double high_thr, int acc_grad, unsigned char *d_edges, int *d_nonzero, cudaStream_t st) {
-  size_t plane = (size_t)nx * ny, n = plane * n_frames;
-  if (n >= (size_t)1 << 31) { set_error("canny: batch of %d frames %dx%d exceeds 2^31 pixels; split the batch", n_frames, nx, ny); return B2F_EUNSUP; }
-  if (!(s > 0)) { set_error("canny: s must be > 0"); return B2F_EINVAL; }
-  const int TX = ceil_div(nx, HT), TY = ceil_div(ny, HT);
-  const size_t tiles = (size_t)TX * TY * n_frames;
-  if (tiles * HYST_MAX_ROOTS >= (size_t)1 << 31) {   // component ids 256*tile + c are int (only very thin frames get here)
-    set_error("canny: batch of %d frames %dx%d has too many 32x32 tiles; split the batch", n_frames, nx, ny);
+// The batch limits of the Canny path: pixel offsets and the component ids 256*tile + c of the hysteresis are int.
+static int canny_batch_geometry(const char *who, int n_frames, int nx, int ny, int *TX, int *TY, int *n_tiles) {
+  if ((size_t)nx * ny * n_frames >= (size_t)1 << 31) {
+    set_error("%s: batch of %d frames %dx%d exceeds 2^31 pixels; split the batch", who, n_frames, nx, ny);
     return B2F_EUNSUP;
   }
-  const int n_tiles = (int)tiles;
-  float *blur = ctx->arena.get<float>(n);
-  unsigned *emask = ctx->arena.get<unsigned>(tiles * HT), *smask = ctx->arena.get<unsigned>(tiles * HT);
+  const size_t tiles = hyst_tile_count(n_frames, nx, ny);
+  if (tiles * HYST_MAX_ROOTS >= (size_t)1 << 31) {   // (only very thin frames get here)
+    set_error("%s: batch of %d frames %dx%d has too many 32x32 tiles; split the batch", who, n_frames, nx, ny);
+    return B2F_EUNSUP;
+  }
+  *TX = ceil_div(nx, HT); *TY = ceil_div(ny, HT); *n_tiles = (int)tiles;
+  return B2F_OK;
+}
+
+// Hysteresis on the tile-major masks emask / smask of n_frames frames (TX x TY tiles each): the edge map (0 / 255) to
+// d_edges and the number of edge pixels per frame to d_nonzero.  Carves its scratch (hyst_scratch_bytes less the masks)
+// from the arena.  Per-component arrays are written by hyst_local for the ids that exist: no memsets.
+static int canny_hysteresis(b2f_ctx *ctx, const unsigned *emask, const unsigned *smask, int n_frames, int nx, int ny, int TX,
+                            int TY, int n_tiles, unsigned char *d_edges, int *d_nonzero, cudaStream_t st) {
+  const size_t tiles = (size_t)n_tiles;
   unsigned char *runc = ctx->arena.get<unsigned char>(tiles * HT * HYST_MAX_RUNS);
   int *ncomp = ctx->arena.get<int>(tiles);
   int *parent = ctx->arena.get<int>(tiles * HYST_MAX_ROOTS);
   unsigned char *strong = ctx->arena.get<unsigned char>(tiles * HYST_MAX_ROOTS), *keep = ctx->arena.get<unsigned char>(tiles * HYST_MAX_ROOTS);
+  B2F_ARENA_CHECK(ctx);
+  B2F_CUDA(cudaMemsetAsync(d_nonzero, 0, sizeof(int) * n_frames, st));
+  const unsigned hb = (unsigned)ceil_div(n_tiles, 8);
+  hyst_local_kernel<<<hb, 256, 0, st>>>(emask, smask, runc, ncomp, parent, strong, n_tiles);
+  B2F_LAUNCH_CHECK(ctx);
+  hyst_seam_kernel<<<hb, 256, 0, st>>>(emask, runc, parent, TX, TY, n_tiles);
+  B2F_LAUNCH_CHECK(ctx);
+  hyst_mark_kernel<<<hb, 256, 0, st>>>(ncomp, parent, strong, n_tiles);
+  B2F_LAUNCH_CHECK(ctx);
+  hyst_resolve_kernel<<<hb, 256, 0, st>>>(ncomp, parent, strong, keep, n_tiles);
+  B2F_LAUNCH_CHECK(ctx);
+  const int vec = (nx % 16 == 0) && ((reinterpret_cast<uintptr_t>(d_edges) & 15) == 0);
+  hyst_emit_kernel<<<hb, 256, 0, st>>>(emask, runc, keep, d_edges, d_nonzero, nx, ny, TX, TY, n_tiles, vec);
+  B2F_LAUNCH_CHECK(ctx);
+  return B2F_OK;
+}
+
+int canny_device(b2f_ctx *ctx, const unsigned char *d_frames, int n_frames, int nx, int ny, double s, double low_thr,
+                 double high_thr, int acc_grad, unsigned char *d_edges, int *d_nonzero, cudaStream_t st) {
+  const size_t n = (size_t)nx * ny * n_frames;
+  int TX, TY, n_tiles;
+  int rc = canny_batch_geometry("canny", n_frames, nx, ny, &TX, &TY, &n_tiles);
+  if (rc != B2F_OK) return rc;
+  if (!(s > 0)) { set_error("canny: s must be > 0"); return B2F_EINVAL; }
+  const size_t tiles = (size_t)n_tiles;
+  float *blur = ctx->arena.get<float>(n);
+  unsigned *emask = ctx->arena.get<unsigned>(tiles * HT), *smask = ctx->arena.get<unsigned>(tiles * HT);
   std::vector<int> cx, cy; std::vector<double> wx, wy;
   make_taps(nx, s, cx, wx); make_taps(ny, s, cy, wy);
   CannyTaps tx, ty;
@@ -956,21 +1013,7 @@ int canny_device(b2f_ctx *ctx, const unsigned char *d_frames, int n_frames, int 
   else
     canny_grad_nms_spec2_kernel<false><<<dim3(TX, TY, n_frames), CG_NT, 0, st>>>(blur, emask, smask, nx, ny, (int)low_thr, (int)high_thr, fc);
   B2F_LAUNCH_CHECK(ctx);
-  B2F_CUDA(cudaMemsetAsync(d_nonzero, 0, sizeof(int) * n_frames, st));
-  // ---- hysteresis on the bit masks; per-component arrays are written by hyst_local for the ids that exist: no memsets
-  const unsigned hb = (unsigned)ceil_div(n_tiles, 8);
-  hyst_local_kernel<<<hb, 256, 0, st>>>(emask, smask, runc, ncomp, parent, strong, n_tiles);
-  B2F_LAUNCH_CHECK(ctx);
-  hyst_seam_kernel<<<hb, 256, 0, st>>>(emask, runc, parent, TX, TY, n_tiles);
-  B2F_LAUNCH_CHECK(ctx);
-  hyst_mark_kernel<<<hb, 256, 0, st>>>(ncomp, parent, strong, n_tiles);
-  B2F_LAUNCH_CHECK(ctx);
-  hyst_resolve_kernel<<<hb, 256, 0, st>>>(ncomp, parent, strong, keep, n_tiles);
-  B2F_LAUNCH_CHECK(ctx);
-  const int vec = (nx % 16 == 0) && ((reinterpret_cast<uintptr_t>(d_edges) & 15) == 0);
-  hyst_emit_kernel<<<hb, 256, 0, st>>>(emask, runc, keep, d_edges, d_nonzero, nx, ny, TX, TY, n_tiles, vec);
-  B2F_LAUNCH_CHECK(ctx);
-  return B2F_OK;
+  return canny_hysteresis(ctx, emask, smask, n_frames, nx, ny, TX, TY, n_tiles, d_edges, d_nonzero, st);
 }
 
 }  // namespace b2f
@@ -998,6 +1041,23 @@ int b2f_canny_dev(b2f_ctx *ctx, const uint8_t *d_frames, int n_frames, int nx, i
   if (rc != B2F_OK) return rc;
   if ((rc = arena_reserve(ctx, canny_scratch_bytes(n_frames, nx, ny))) != B2F_OK) return rc;
   return canny_device(ctx, d_frames, n_frames, nx, ny, s, low_thr, high_thr, acc_grad, d_edges, d_nonzero, st);
+}
+
+int b2f_canny_hysteresis_dev(b2f_ctx *ctx, const uint8_t *d_cls, int n_frames, int nx, int ny, uint8_t *d_edges,
+                             int *d_nonzero, void *stream) {
+  if (!ctx || !d_cls || !d_edges || !d_nonzero || n_frames <= 0 || nx <= 0 || ny <= 0) { set_error("b2f_canny_hysteresis_dev: bad argument"); return B2F_EINVAL; }
+  int TX, TY, n_tiles;
+  int rc = canny_batch_geometry("b2f_canny_hysteresis_dev", n_frames, nx, ny, &TX, &TY, &n_tiles);
+  if (rc != B2F_OK) return rc;
+  B2F_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st;
+  if ((rc = stream_handoff(ctx, stream, &st)) != B2F_OK) return rc;
+  if ((rc = arena_reserve(ctx, hyst_scratch_bytes((size_t)n_tiles))) != B2F_OK) return rc;
+  unsigned *emask = ctx->arena.get<unsigned>((size_t)n_tiles * HT), *smask = ctx->arena.get<unsigned>((size_t)n_tiles * HT);
+  B2F_ARENA_CHECK(ctx);
+  hyst_pack_kernel<<<dim3(TX, TY, n_frames), 256, 0, st>>>(d_cls, emask, smask, nx, ny);
+  B2F_LAUNCH_CHECK(ctx);
+  return canny_hysteresis(ctx, emask, smask, n_frames, nx, ny, TX, TY, n_tiles, d_edges, d_nonzero, st);
 }
 
 int b2f_canny_batch(b2f_ctx *ctx, const uint8_t *frames, int n_frames, int nx, int ny, double s, double low_thr,

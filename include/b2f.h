@@ -120,6 +120,11 @@ int b2f_canny_batch(b2f_ctx *ctx, const uint8_t *frames, int n_frames, int nx, i
 int b2f_canny_dev(b2f_ctx *ctx, const uint8_t *d_frames, int n_frames, int nx, int ny, double s,
                   double low_thr, double high_thr, int acc_grad, uint8_t *d_edges, int *d_nonzero,
                   void *stream);
+/* Canny hysteresis on given class maps (the stage after NMS): d_cls = n_frames*ny*nx bytes; a pixel is an edge
+ * candidate iff its byte is non-zero and strong iff it is 2 (rcpp_canny.cpp:184-215).  Output as b2f_canny_dev.
+ * Runs the same hysteresis kernels as b2f_canny_dev (stage-level testing). */
+int b2f_canny_hysteresis_dev(b2f_ctx *ctx, const uint8_t *d_cls, int n_frames, int nx, int ny,
+                             uint8_t *d_edges, int *d_nonzero, void *stream);
 
 /* pixels of this context's Canny calls that the fp32 tier could not certify and the exact fp64 tier decided (since b2f_init) */
 int b2f_canny_stats(b2f_ctx *ctx, unsigned long long *tier2_pixels);

@@ -149,6 +149,17 @@ def canny(img, s=2.0, low_thr=3.0, high_thr=10.0, accGrad=True, impl="oracle", s
     return e, nz
 
 
+def canny_hysteresis(cls):
+    """Hysteresis alone (orc_canny_hysteresis, a flood fill from the class-2 seeds) on a class map uint8 [ny, nx]
+    (0 = no edge, 2 = strong, any other value = weak).  Returns (edges uint8 0/255 [ny, nx], number of edge pixels)."""
+    c = np.ascontiguousarray(cls, dtype=np.uint8)
+    ny, nx = c.shape
+    e = np.zeros((ny, nx), np.uint8)
+    fn = lib("oracle").orc_canny_hysteresis; fn.restype = C.c_int
+    nz = fn(_p(c), nx, ny, _p(e))
+    return e, nz
+
+
 def canny_blur_ref(img, s):
     """The reference's own gblur (tools.c) through the DFT shim: float-rounded doubles."""
     a = np.ascontiguousarray(img, dtype=np.float64)

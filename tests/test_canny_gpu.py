@@ -73,6 +73,89 @@ def test_int_narrowing_like_reference(oracle):
     assert out["pixels_nonzero"] == cnt and np.array_equal(out["edges"].T == 255, e == 255)
 
 
+def _check_batch(oracle, frames, edges, nz, **kw):
+    for i in range(frames.shape[0]):
+        e, cnt = oracle.canny(frames[i], **kw)
+        assert int(nz[i]) == cnt, (i, int(nz[i]), cnt)
+        assert np.array_equal(edges[i], e), "frame %d: %d mismatching pixels" % (i, int((edges[i] != e).sum()))
+
+
+def test_spiral_long_weak_chains(oracle):
+    """A spiral whose contrast fades outwards: each arm is one weak chain over >= 50 tiles, seeded in one tile."""
+    import hyst_maps as H
+    from image_b200.canny import canny_batch
+    img = H.spiral_image()
+    assert H.longest_single_seed_span(oracle.canny(img, stages=True)[3]) >= 50
+    frames = np.stack([img, img[::-1, ::-1].copy()])
+    edges, nz = canny_batch(frames)
+    _check_batch(oracle, frames, edges, nz)
+
+
+def test_diagonal_stripes_cross_tile_corners(oracle):
+    """45-degree stripes of period 32 whose edge lines pass diagonally through tile corners; the strong heads of
+    the lines reach their weak tails only through those corners (bottom-right and bottom-left kinds)."""
+    import hyst_maps as H
+    from image_b200.canny import canny_batch
+    frames = np.stack([H.diagonal_stripes(anti=False), H.diagonal_stripes(anti=True)])
+    for f, keep in zip(frames, [("bl",), ("br",)]):
+        c = oracle.canny(f, stages=True)[3]
+        assert not np.array_equal(H.graph_hysteresis(c)[0], H.graph_hysteresis(c, corners=keep)[0])
+    edges, nz = canny_batch(frames)
+    _check_batch(oracle, frames, edges, nz)
+
+
+def test_fine_grating_many_runs_per_row(oracle):
+    """A period-3 grating with low thresholds: tile rows of the NMS masks with 10 and more runs."""
+    import hyst_maps as H
+    from image_b200.canny import canny_batch
+    img = H.fine_grating()
+    kw = dict(s=1.0, low_thr=1.0, high_thr=5.0)
+    assert H.max_runs_per_row(oracle.canny(img, stages=True, **kw)[3]) >= 10
+    frames = np.stack([img, img[:, ::-1].copy()])
+    edges, nz = canny_batch(frames, **kw)
+    _check_batch(oracle, frames, edges, nz, **kw)
+
+
+CORNER_TIE = pytest.mark.xfail(strict=True, reason=(
+    "NMS tier 2 forms the direction cosines as h/|g|, not as the reference's cos(atan2(v, h)); at an image corner whose "
+    "gradient points out of the image the clamped bilinear neighbour is the pixel itself, so `now <= neighbour` is a "
+    "rounding tie that the last bit of the cosine decides (frame 26 here: pixel (19, 0) is class 2 in the reference, 0 on "
+    "the GPU)"))
+
+
+@pytest.mark.parametrize("shape", [pytest.param((20, 20), marks=CORNER_TIE), (33, 33), (40, 1), (7, 5)])
+def test_many_tiny_frames_in_one_call(oracle, shape):
+    """About 40 distinct tiny frames in one call: one hysteresis CTA covers several frames (2, 4 and 8 of them for the
+    last three shapes), whose counts it must split."""
+    from image_b200.canny import canny_batch
+    rng = np.random.default_rng(shape[0] * 100 + shape[1])
+    frames = rng.integers(0, 256, (41,) + shape).astype(np.uint8)
+    frames[::7] = 90                                        # some flat frames: no edges between edged ones
+    frames[3::7] //= 8                                      # some low-contrast ones
+    edges, nz = canny_batch(frames, low_thr=2.0, high_thr=30.0)
+    _check_batch(oracle, frames, edges, nz, low_thr=2.0, high_thr=30.0)
+    assert len(set(nz.tolist())) > 5
+
+
+def test_canny_dev_misaligned_edges(oracle):
+    """canny_dev into an edge map that is not 16-byte aligned although nx % 16 == 0 (the scalar stores of the emit
+    kernel), inside a guard buffer that must stay untouched."""
+    import torch
+    from image_b200 import synth
+    from image_b200.canny import canny_dev
+    frames = np.stack([synth.frame_shapes(640 + i, 96, 128) for i in range(3)])
+    size, guard, sent = frames.size, 4096, 0x5A
+    d_frames = torch.from_numpy(frames).cuda()
+    buf = torch.full((size + 2 * guard + 16,), sent, dtype=torch.uint8, device="cuda")
+    nz = torch.full((3,), -1, dtype=torch.int32, device="cuda")
+    torch.cuda.synchronize()
+    canny_dev(d_frames, 3, 128, 96, buf.data_ptr() + guard + 1, nz)
+    torch.cuda.synchronize()
+    b = buf.cpu().numpy()
+    assert (b[:guard + 1] == sent).all() and (b[guard + 1 + size:] == sent).all()
+    _check_batch(oracle, frames, b[guard + 1:guard + 1 + size].reshape(frames.shape), nz.cpu().numpy())
+
+
 def test_hysteresis_properties_full_hd_batch():
     """BASELINE config 2 size (1920x1080): size-independent properties — idempotent batch entries,
     every strong seed survives, raising the low threshold can only remove pixels."""
