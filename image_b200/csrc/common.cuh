@@ -72,6 +72,7 @@ struct b2f_ctx {
   void *harris_stats = nullptr;   // device PatchStats (harris.cu): certification counters since the context was created
   void *surf_gauss = nullptr; // 109 Gaussian weights of the SURF orientation samples (surf.cu), built on first use
   void *fhog_lut = nullptr;   // 511x511 orientation-snap table (fhog.cu), built on first use
+  void *nlmeans_lut = nullptr;   // 30000-entry exp(-x) table of NL-means (nlmeans.cu), uploaded on first use
   // FHOG vote tables of the last geometry (fhog.cu): one device block, rebuilt when (rows, cols, cell) changes
   void *fhog_tab = nullptr;
   size_t fhog_tab_cap = 0;

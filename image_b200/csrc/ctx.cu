@@ -172,6 +172,7 @@ void b2f_shutdown(b2f_ctx *c) {
   if (c->harris_stats) cudaFree(c->harris_stats);
   if (c->surf_gauss) cudaFree(c->surf_gauss);
   if (c->fhog_lut) cudaFree(c->fhog_lut);
+  if (c->nlmeans_lut) cudaFree(c->nlmeans_lut);
   if (c->fhog_tab) cudaFree(c->fhog_tab);
   if (c->s_in) { cudaStreamSynchronize(c->s_in); cudaStreamDestroy(c->s_in); }
   if (c->s_out) { cudaStreamSynchronize(c->s_out); cudaStreamDestroy(c->s_out); }

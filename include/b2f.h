@@ -247,6 +247,27 @@ int b2f_otsu_batch_u8(b2f_ctx *ctx, const uint8_t *frames, int n_frames, int wid
 int b2f_otsu_dev(b2f_ctx *ctx, const uint8_t *d_frames, int n_frames, int width, int height, int override_threshold,
                  uint8_t *d_out, int *d_thresholds, void *stream);
 
+/* ---------------------------------------------------------------------------- NL-means ----
+ * Non-local means of image.DenoiseNLMeans (rcpp_nlmeans, image.DenoiseNLMeans/src/rcpp_denoisenlmeans.cpp, which calls
+ * nlmeans_ipol in libdenoising.cpp).  Images are channel-planar: value x + width*y + width*height*c.  Output values are
+ * the reference's float results bit for bit, in the order the reference computes them when run on one thread (DESIGN.md
+ * §5: its OpenMP loop races on the output).  channels is mapped like the glue: 2 -> 1, above 3 -> 3; 0 or below is an error.
+ * b2f_nlmeans_resolve: the glue's parameter table.  With args_auto != 0, (*win, *bloc, *filter) are set from the row of
+ *   `channels` (1 = grey, else colour) and sigma; sigma <= 0 takes the last row, sigma > 100 (or NaN) returns B2F_EINVAL
+ *   with the reference's message.  With args_auto == 0 the values are left as given.  Host code only, no context.
+ * b2f_nlmeans_host_r32: the body of rcpp_nlmeans.  image = width*height*channels R integers, narrowed to float on the
+ *   device; three equal planes are denoised as one (*out_channels = 1).  out receives *out_channels planes of floats
+ *   (room for width*height*min(mapped channels) is needed); *_used are the parameters the call ran with.
+ * b2f_nlmeans_dev: n_frames u8 frames [n][channels][height][width] in HBM -> d_out float [n][C][height][width] with
+ *   C the mapped channel count, explicit parameters, no colour test.  One launch sequence for the whole batch,
+ *   asynchronous on `stream` (NULL = ctx stream). */
+int b2f_nlmeans_resolve(int channels, float sigma, int args_auto, int *win, int *bloc, float *filter);
+int b2f_nlmeans_host_r32(b2f_ctx *ctx, const int32_t *image, int width, int height, int channels, float sigma, int args_auto,
+                         int win, int bloc, float filter, float *out, int *out_channels, int *win_used, int *bloc_used,
+                         float *filter_used);
+int b2f_nlmeans_dev(b2f_ctx *ctx, const uint8_t *d_frames, int n_frames, int channels, int width, int height, int win, int bloc,
+                    float sigma, float filter, float *d_out, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
