@@ -84,7 +84,12 @@ lsd_gradient_kernel(const double *__restrict__ in, double *__restrict__ angles, 
 
 // The ordered list is a stable counting sort of the (N-1)(M-1) gradient pixels, visited x outer / y inner, by bucket
 // (highest first).  Sequence position s <-> (x = s / (M-1), y = s % (M-1)).
+// A frame without a defined angle keeps max_grad == 0, and the reference's quotient is NaN (norm 0) or +inf.  Its
+// (unsigned) conversion is undefined in C; the x86-64 build truncates through a signed 64-bit integer, which gives
+// INT64_MIN, low 32 bits 0: every pixel lands in bucket 0 (DESIGN.md §5).  That is decided here, not left to the
+// device's conversion (sm_90 gives 0x80000000 for NaN and 0xFFFFFFFF for +inf: one clamped bucket too, by accident).
 __device__ __forceinline__ int lsd_bucket(double norm, double max_grad, int n_bins) {     // lsd.c:844-845
+  if (!(max_grad > 0.0)) return 0;
   unsigned i = (unsigned)__ddiv_rn(__dmul_rn(norm, (double)n_bins), max_grad);
   return i >= (unsigned)n_bins ? n_bins - 1 : (int)i;
 }
