@@ -107,6 +107,11 @@ def load():
         ("b2f_nlmeans_resolve", [C.c_int, C.c_float, C.c_int, ip, ip, fp]),
         ("b2f_nlmeans_host_r32", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, C.c_float, vp, ip, ip, ip, fp]),
         ("b2f_nlmeans_dev", [vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, vp, vp]),
+        ("b2f_facedet_model_create", [vp, vp, C.c_int, C.POINTER(vp)]),
+        ("b2f_facedet_model_free", [vp]),
+        ("b2f_facedet_host_r32", [vp, vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, ip, vp]),
+        ("b2f_facedet_batch_rgb", [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp]),
+        ("b2f_facedet_dev", [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp]),
     ]:
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
@@ -177,4 +182,5 @@ EXPORTS = [
     "b2f_harris_host_r64", "b2f_canny_host_r32", "b2f_fhog_host_r32", "b2f_surf_host_r32", "b2f_features_batch_rgb", "b2f_features_batch_grey", "b2f_lsd_front_size", "b2f_lsd_front_host", "b2f_lsd_front_dev",
     "b2f_contour_edge_points_host", "b2f_contour_edge_points_batch_u8", "b2f_contour_edge_points_dev",
     "b2f_nlmeans_resolve", "b2f_nlmeans_host_r32", "b2f_nlmeans_dev",
+    "b2f_facedet_model_create", "b2f_facedet_model_free", "b2f_facedet_host_r32", "b2f_facedet_batch_rgb", "b2f_facedet_dev",
 ]

@@ -268,6 +268,43 @@ int b2f_nlmeans_host_r32(b2f_ctx *ctx, const int32_t *image, int width, int heig
 int b2f_nlmeans_dev(b2f_ctx *ctx, const uint8_t *d_frames, int n_frames, int channels, int width, int height, int win, int bloc,
                     float sigma, float filter, float *d_out, void *stream);
 
+/* ---------------------------------------------------------------------- face detection ----
+ * The CNN face detector of image.libfacedetection (detect_faces, src/rcpp_libfacedetection.cpp, which calls facedetect_cnn
+ * in facedetectcnn-model.cpp).  Detections are the reference's bit for bit, as gcc -O2 builds it on x86-64 (DESIGN.md §5).
+ * The library ships no weights: the model is built from the R package's own table.
+ * b2f_conv_layer: the layout of the reference's ConvInfoStruct, so its param_pConvInfo[24] can be passed as it is.
+ *   weights are [num][channels][kernel_size][kernel_size].
+ * b2f_facedet_model_create: checks the 24 layers against the network (shapes; stride 1 and pad 1 / 0 for the 3x3 / 1x1
+ *   layers 1..23; layer 0 is 3x3 over 3 colours to 32 channels) and returns B2F_EINVAL with a message for anything else;
+ *   repacks the weights once into device memory of ctx's device.  Released by b2f_facedet_model_free.
+ * Faces are int32 [256][15] per frame: confidence, x, y, width, height, then the five landmark (x, y) pairs, after the
+ *   reference's short casts; *n_faces (<= 100) of them are set, the rest are 0.
+ * b2f_facedet_host_r32: the body of detect_faces.  x = x_len R integers, the interleaved RGB frame row by row (R's
+ *   aperm(x, c(3, 2, 1))), narrowed like the glue's (unsigned char) cast.  step must be 3 * width and x_len at least
+ *   3 * width * height (B2F_EINVAL otherwise); width or height <= 0 gives 0 faces, as in the reference.
+ * b2f_facedet_batch_rgb: n_frames host frames [n][height][width][3] u8 -> n_faces [n], faces [n][256][15]; chunked, with the
+ *   upload of the next chunk overlapping the current one.
+ * b2f_facedet_dev: the same for frames in HBM, on `stream` (NULL = ctx stream); returns when the host outputs are written.
+ *   Optional outputs: layer_max [n][16] = the per-frame maximum of each ReLU layer after the ReLU (-1 for a layer the
+ *   reference does not run on a frame this small), and the candidate records the head pass sends to the host tail:
+ *   cand [n][cand_cap][17] = (prior index in the reference's concatenation order, 2 conf ints, 14 loc ints) sorted by
+ *   prior index, n_cand [n] = their number (records beyond cand_cap are counted but not written). */
+typedef struct b2f_conv_layer {
+  int pad, stride, kernel_size, channels, num;
+  float scale;
+  const int8_t *weights;
+  const int32_t *bias;
+} b2f_conv_layer;
+typedef struct b2f_facedet_model b2f_facedet_model;
+int b2f_facedet_model_create(b2f_ctx *ctx, const b2f_conv_layer *layers, int n_layers, b2f_facedet_model **model);
+void b2f_facedet_model_free(b2f_facedet_model *model);
+int b2f_facedet_host_r32(b2f_ctx *ctx, const b2f_facedet_model *model, const int32_t *x, size_t x_len, int width, int height,
+                         int step, int *n_faces, int32_t *faces);
+int b2f_facedet_batch_rgb(b2f_ctx *ctx, const b2f_facedet_model *model, const uint8_t *frames, int n_frames, int width, int height,
+                          int *n_faces, int32_t *faces);
+int b2f_facedet_dev(b2f_ctx *ctx, const b2f_facedet_model *model, const uint8_t *d_frames, int n_frames, int width, int height,
+                    int *n_faces, int32_t *faces, int32_t *layer_max, int32_t *cand, int cand_cap, int *n_cand, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
