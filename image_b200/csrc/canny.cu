@@ -1063,41 +1063,9 @@ int b2f_canny_hysteresis_dev(b2f_ctx *ctx, const uint8_t *d_cls, int n_frames, i
 int b2f_canny_batch(b2f_ctx *ctx, const uint8_t *frames, int n_frames, int nx, int ny, double s, double low_thr,
                     double high_thr, int acc_grad, uint8_t *edges, int *nonzero) {
   if (!ctx || !frames || !edges || !nonzero || n_frames <= 0 || nx <= 0 || ny <= 0) { set_error("b2f_canny_batch: bad argument"); return B2F_EINVAL; }
-  B2F_CUDA(cudaSetDevice(ctx->device));
-  const size_t plane = (size_t)nx * ny, n = plane * n_frames;
-  const int C = frames_per_chunk(ctx, plane, n_frames), NCH = ceil_div(n_frames, C);
-  int rc = arena_reserve(ctx, canny_scratch_bytes(C, nx, ny) + 2 * align256(n) + align256(n_frames * 4));
-  if (rc != B2F_OK) return rc;
-  unsigned char *d_in = ctx->arena.get<unsigned char>(n), *d_out = ctx->arena.get<unsigned char>(n);
-  int *d_nz = ctx->arena.get<int>(n_frames);
-  B2F_ARENA_CHECK(ctx);
-  const size_t mark = ctx->arena.off;
-  cudaStream_t st = ctx->stream;
-  if ((rc = pipe_prepare(ctx, 2 * NCH)) != B2F_OK) return rc;
-  for (int c = 0; c < NCH; c++) {          // upload c+1 | kernels c | download c-1 overlap
-    const int f0 = c * C, nf = std::min(C, n_frames - f0);
-    cudaEvent_t e_in = ctx->events[2 * c], e_done = ctx->events[2 * c + 1];
-    rc = B2F_OK;
-    if (cudaMemcpyAsync(d_in + plane * f0, frames + plane * f0, plane * nf, cudaMemcpyHostToDevice, ctx->s_in) != cudaSuccess ||
-        cudaEventRecord(e_in, ctx->s_in) != cudaSuccess || cudaStreamWaitEvent(st, e_in, 0) != cudaSuccess) rc = B2F_ECUDA;
-    ctx->arena.off = mark;
-    if (rc == B2F_OK) rc = canny_device(ctx, d_in + plane * f0, nf, nx, ny, s, low_thr, high_thr, acc_grad, d_out + plane * f0, d_nz + f0, st);
-    if (rc == B2F_OK && (cudaEventRecord(e_done, st) != cudaSuccess || cudaStreamWaitEvent(ctx->s_out, e_done, 0) != cudaSuccess ||
-                         cudaMemcpyAsync(edges + plane * f0, d_out + plane * f0, plane * nf, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess)) rc = B2F_ECUDA;
-    if (rc != B2F_OK) {
-      if (rc == B2F_ECUDA) set_error("b2f_canny_batch: CUDA error in chunk %d: %s", c, cudaGetErrorString(cudaGetLastError()));
-      pipe_drain(ctx);
-      return rc;
-    }
-  }
-  // the counters go last: `nonzero` is usually pageable memory, and a copy into pageable memory blocks the
-  // host until the stream reaches it -- inside the loop it would serialise the chunks
-  if (cudaMemcpyAsync(nonzero, d_nz, sizeof(int) * n_frames, cudaMemcpyDeviceToHost, st) != cudaSuccess) {
-    set_error("b2f_canny_batch: %s", cudaGetErrorString(cudaGetLastError()));
-    pipe_drain(ctx);
-    return B2F_ECUDA;
-  }
-  return pipe_drain(ctx);
+  const b2f_canny_params cp = {s, low_thr, high_thr, acc_grad};
+  return features_batch("b2f_canny_batch", ctx, frames, 1, n_frames, ny, nx, nullptr, 0, nullptr, nullptr, nullptr, nullptr,
+                        &cp, edges, nonzero, 0, 0, 0, nullptr);
 }
 
 int b2f_canny_host(b2f_ctx *ctx, const uint8_t *img, int nx, int ny, double s, double low_thr, double high_thr,

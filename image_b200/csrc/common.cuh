@@ -100,6 +100,12 @@ int pinned_reserve_aux(b2f_ctx *ctx, int which, size_t bytes);   // grows block 
 int stream_handoff(b2f_ctx *ctx, void *user_stream, cudaStream_t *out);
 int pipe_prepare(b2f_ctx *ctx, int n_events);
 int pipe_drain(b2f_ctx *ctx);                       // wait for all three streams (also used on error paths)
+// The host-batch pipeline of Harris, Canny and FHOG (features.cu), for any subset of them: hp = NULL, cp = NULL or
+// cell_size = 0 skips a detector.  channels = 3: interleaved RGB frames (grey derived on the device); 1: grey frames
+// (no FHOG).  `who` names the public entry point in error messages.
+int features_batch(const char *who, b2f_ctx *ctx, const uint8_t *frames, int channels, int n_frames, int rows, int cols,
+                   const b2f_harris_params *hp, int corner_cap, float *cx, float *cy, float *cs, int *ccounts,
+                   const b2f_canny_params *cp, uint8_t *edges, int *nonzero, int cell_size, int frp, int fcp, float *hog);
 inline int frames_per_chunk(const b2f_ctx *ctx, size_t frame_bytes, int n_frames) {
   const size_t target = ctx->chunk_bytes;
   size_t c = target / (frame_bytes ? frame_bytes : 1);

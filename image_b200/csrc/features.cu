@@ -4,6 +4,8 @@
 // plane both Harris and Canny read is derived on the device with dlib's rule (r + g + b) / 3 (pixel.h:775-783 — the
 // same grey the reference's SURF path uses, and what bench.py feeds the single-detector calls).  Frames are cut into
 // chunks; the upload of chunk c+1, the kernels of chunk c and the download of chunk c-1 overlap on three streams.
+// The single-detector host batches (b2f_harris_batch_u8, b2f_canny_batch, b2f_fhog_batch) run this same pipeline with
+// one detector.
 #include "harris_host.h"
 #include <algorithm>
 #include <chrono>
@@ -42,24 +44,19 @@ rgb_to_grey_kernel(const unsigned char *__restrict__ rgb, unsigned char *__restr
     for (size_t j = i; j < e; j++) grey[j] = (unsigned char)(((unsigned)rgb[3 * j] + rgb[3 * j + 1] + rgb[3 * j + 2]) / 3);
   }
 }
-}  // namespace b2f
 
-using namespace b2f;
-
-// channels = 3: interleaved RGB frames (grey derived on the device); channels = 1: grey frames (no FHOG)
-static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_frames, int rows, int cols,
-                          const b2f_harris_params *hp, int corner_cap, float *cx, float *cy, float *cs, int *ccounts,
-                          const b2f_canny_params *cp, uint8_t *edges, int *nonzero,
-                          int cell_size, int frp, int fcp, float *hog) {
-  if (!ctx || !rgb || n_frames <= 0 || rows <= 0 || cols <= 0) { set_error("b2f_features_batch_rgb: bad argument"); return B2F_EINVAL; }
+int features_batch(const char *who, b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_frames, int rows, int cols,
+                   const b2f_harris_params *hp, int corner_cap, float *cx, float *cy, float *cs, int *ccounts,
+                   const b2f_canny_params *cp, uint8_t *edges, int *nonzero, int cell_size, int frp, int fcp, float *hog) {
+  if (!ctx || !rgb || n_frames <= 0 || rows <= 0 || cols <= 0) { set_error("%s: bad argument", who); return B2F_EINVAL; }
   const bool do_h = hp != nullptr, do_c = cp != nullptr, do_f = cell_size > 0;
-  if (do_h && (!cx || !cy || !cs || !ccounts || corner_cap <= 0)) { set_error("b2f_features_batch_rgb: Harris outputs missing"); return B2F_EINVAL; }
-  if (do_h && (hp->strategy != 0 || hp->precision != 0 || hp->Nscales > 1)) { set_error("b2f_features_batch_rgb: corners come in raster order (strategy=0, precision=0, Nscales=1)"); return B2F_EUNSUP; }
-  if (do_c && (!edges || !nonzero)) { set_error("b2f_features_batch_rgb: Canny outputs missing"); return B2F_EINVAL; }
+  if (do_h && (!cx || !cy || !cs || !ccounts || corner_cap <= 0)) { set_error("%s: Harris outputs missing", who); return B2F_EINVAL; }
+  if (do_h && (hp->strategy != 0 || hp->precision != 0 || hp->Nscales > 1)) { set_error("%s: corners come in raster order (strategy=0, precision=0, Nscales=1)", who); return B2F_EUNSUP; }
+  if (do_c && (!edges || !nonzero)) { set_error("%s: Canny outputs missing", who); return B2F_EINVAL; }
   int hnr = 0, hnc = 0, rc;
   if (do_f) {
-    if ((rc = fhog_check_args("b2f_features_batch_rgb", rows, cols, cell_size, frp, fcp)) != B2F_OK) return rc;
-    if (!hog) { set_error("b2f_features_batch_rgb: FHOG output missing"); return B2F_EINVAL; }
+    if ((rc = fhog_check_args(who, rows, cols, cell_size, frp, fcp)) != B2F_OK) return rc;
+    if (!hog) { set_error("%s: FHOG output missing", who); return B2F_EINVAL; }
   }
   const auto t_enter = std::chrono::steady_clock::now();
   B2F_CUDA(cudaSetDevice(ctx->device));
@@ -83,20 +80,21 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
   const int NCH = (int)cstart.size() - 1;
   const size_t f_scr = do_f ? fhog_scratch_simple(C, rows, cols, cell_size, frp, fcp, &hnr, &hnc) : 0;
   const size_t fout = (size_t)hnr * hnc * 31;
+  // Harris scratch only where some pixel has a full window (harris_corners_device zeroes the counts of other frames)
   const int radius = do_h ? (int)(2 * hp->sigma_i + 0.5) : 0;
   const bool h_runs = do_h && !(nx < 3 || ny < 3 || ny <= 2 * radius + 1 || nx <= 2 * radius + 1);
-  const bool certified = h_runs && hp->exact == 0 && harris_certified_supported(nx, ny, hp);
+  const bool derive_grey = channels == 3 && (do_h || do_c);
   // the detectors run side by side on three streams: each has its own scratch region
   const size_t scr_h = h_runs ? align256(harris_scratch_bytes(C, nx, ny, hp, corner_cap)) : 0;
   const size_t scr_c = do_c ? align256(canny_scratch_bytes(C, nx, ny)) : 0;
   const size_t scr = scr_h + scr_c + align256(f_scr);
   const size_t rec = (size_t)n_frames * corner_cap;
-  rc = arena_reserve(ctx, scr + align256(fin * n_frames) + 2 * align256(plane * C) + (do_c ? align256(plane * n_frames) : 0) + align256(fout * n_frames * 4) +
-                              2 * align256(rec * 4) + 2 * align256((size_t)n_frames * 4) + 8192);
+  rc = arena_reserve(ctx, scr + align256(fin * n_frames) + (derive_grey ? 2 * align256(plane * C) : 0) + (do_c ? align256(plane * n_frames) : 0) +
+                              align256(fout * n_frames * 4) + 2 * align256(rec * 4) + 2 * align256((size_t)n_frames * 4) + 8192);
   if (rc != B2F_OK) return rc;
   unsigned char *d_rgb = ctx->arena.get<unsigned char>(fin * n_frames);
   unsigned char *d_grey2[2] = {nullptr, nullptr};   // derived grey planes of one chunk, double-buffered (Canny of chunk c reads while chunk c+1 is derived)
-  if (channels == 3) { d_grey2[0] = ctx->arena.get<unsigned char>(plane * C); d_grey2[1] = ctx->arena.get<unsigned char>(plane * C); }
+  if (derive_grey) { d_grey2[0] = ctx->arena.get<unsigned char>(plane * C); d_grey2[1] = ctx->arena.get<unsigned char>(plane * C); }
   unsigned char *d_edges = do_c ? ctx->arena.get<unsigned char>(plane * n_frames) : nullptr;
   float *d_hog = do_f && fout ? ctx->arena.get<float>(fout * n_frames) : nullptr;
   int *d_xy = do_h ? ctx->arena.get<int>(rec) : nullptr;
@@ -108,7 +106,6 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
   for (cudaStream_t &s : ctx->s_aux)
     if (!s) B2F_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
   cudaStream_t s_canny = ctx->s_aux[0], s_fhog = ctx->s_aux[1];
-  if (do_h && !h_runs) B2F_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(int) * n_frames, st));
   // The head of every corner list (SPEC entries) and the counters ride home with their chunk, into pinned memory, so the
   // usual case (a few thousand corners per frame) needs no second round trip after the pipeline has drained.
   const int SPEC = std::min(corner_cap, 4096);
@@ -152,7 +149,7 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
       if (rc == B2F_OK && (cudaEventRecord(e_hog, s_fhog) != cudaSuccess || cudaStreamWaitEvent(ctx->s_out, e_hog, 0) != cudaSuccess ||
                            cudaMemcpyAsync(hog + fout * f0, d_hog + fout * f0, fout * nf * 4, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess)) rc = B2F_ECUDA;
     }
-    if (rc == B2F_OK && (do_h || do_c) && channels == 3) {
+    if (rc == B2F_OK && derive_grey) {
       const size_t npx = plane * nf;
       const int al = ((reinterpret_cast<uintptr_t>(d_rgb + fin * f0) | reinterpret_cast<uintptr_t>(d_grey)) & 15) == 0;
       if (do_c && c >= 2 && cudaStreamWaitEvent(st, ctx->events[5 * (c - 2) + 2], 0) != cudaSuccess) rc = B2F_ECUDA;   // Canny of chunk c-2 read this buffer
@@ -168,15 +165,10 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
                            cudaMemcpyAsync(edges + plane * f0, d_edges + plane * f0, plane * nf, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess ||
                            cudaMemcpyAsync(p_nz + f0, d_nz + f0, sizeof(int) * nf, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess)) rc = B2F_ECUDA;
     }
-    if (rc == B2F_OK && h_runs) {
+    if (rc == B2F_OK && do_h) {
       ctx->arena.region(mark_h, mark_c);
-      if (certified) rc = harris_corners_certified(ctx, d_grey_c, true, nf, nx, ny, hp, corner_cap, d_xy + (size_t)f0 * corner_cap, d_s + (size_t)f0 * corner_cap, nullptr, d_cnt + f0, nullptr, st);
-      else {
-        float *d_R = ctx->arena.get<float>(plane * nf);
-        if (!d_R) { set_error("internal: scratch arena under-reserved in b2f_features_batch_rgb"); rc = B2F_ENOMEM; }
-        if (rc == B2F_OK) rc = harris_response_device(ctx, d_grey_c, true, nf, nx, ny, hp, hp->exact == 2 ? 0 : 1, d_R, st);
-        if (rc == B2F_OK) rc = harris_nms_device(ctx, d_R, nf, nx, ny, hp->threshold, radius, corner_cap, d_xy + (size_t)f0 * corner_cap, d_s + (size_t)f0 * corner_cap, d_cnt + f0, st);
-      }
+      rc = harris_corners_device(ctx, d_grey_c, true, nf, nx, ny, hp, corner_cap, d_xy + (size_t)f0 * corner_cap, d_s + (size_t)f0 * corner_cap,
+                                 d_cnt + f0, nullptr, st);
     }
     if (rc == B2F_OK && (cudaEventRecord(e_done, st) != cudaSuccess || cudaStreamWaitEvent(ctx->s_out, e_done, 0) != cudaSuccess)) rc = B2F_ECUDA;
     if (trace) cudaEventRecord(tev[3 + 4 * c], st);
@@ -186,7 +178,7 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
     if (rc == B2F_OK && do_h && cudaMemcpyAsync(p_cnt + f0, d_cnt + f0, sizeof(int) * nf, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess) rc = B2F_ECUDA;
     if (trace) cudaEventRecord(tev[4 + 4 * c], ctx->s_out);
     if (rc != B2F_OK) {
-      if (rc == B2F_ECUDA) set_error("b2f_features_batch_rgb: CUDA error in chunk %d: %s", c, cudaGetErrorString(cudaGetLastError()));
+      if (rc == B2F_ECUDA) set_error("%s: CUDA error in chunk %d: %s", who, c, cudaGetErrorString(cudaGetLastError()));
       pipe_drain(ctx);
       return rc;
     }
@@ -233,9 +225,13 @@ static int features_batch(b2f_ctx *ctx, const uint8_t *rgb, int channels, int n_
       for (int i = SPEC; i < m; i++) { const int q = h_xy[o + i]; cx[o + i] = (float)(q % nx); cy[o + i] = (float)(q / nx); cs[o + i] = h_s[o + i]; }
     }
   }
-  if (over) { set_error("b2f_features_batch_rgb: at least one frame has more than corner_cap=%d corners", corner_cap); return B2F_ECAP; }
+  if (over) { set_error("%s: at least one frame has more than corner_cap=%d corners", who, corner_cap); return B2F_ECAP; }
   return B2F_OK;
 }
+
+}  // namespace b2f
+
+using namespace b2f;
 
 extern "C" {
 
@@ -243,14 +239,16 @@ int b2f_features_batch_rgb(b2f_ctx *ctx, const uint8_t *rgb, int n_frames, int r
                            const b2f_harris_params *hp, int corner_cap, float *cx, float *cy, float *cs, int *ccounts,
                            const b2f_canny_params *cp, uint8_t *edges, int *nonzero,
                            int cell_size, int frp, int fcp, float *hog) {
-  return features_batch(ctx, rgb, 3, n_frames, rows, cols, hp, corner_cap, cx, cy, cs, ccounts, cp, edges, nonzero, cell_size, frp, fcp, hog);
+  return features_batch("b2f_features_batch_rgb", ctx, rgb, 3, n_frames, rows, cols, hp, corner_cap, cx, cy, cs, ccounts, cp, edges, nonzero,
+                        cell_size, frp, fcp, hog);
 }
 
 // grey u8 frames [n][ny][nx]: Harris corners + Canny edge map from one upload (BASELINE.json config 5's stream)
 int b2f_features_batch_grey(b2f_ctx *ctx, const uint8_t *grey, int n_frames, int nx, int ny,
                             const b2f_harris_params *hp, int corner_cap, float *cx, float *cy, float *cs, int *ccounts,
                             const b2f_canny_params *cp, uint8_t *edges, int *nonzero) {
-  return features_batch(ctx, grey, 1, n_frames, ny, nx, hp, corner_cap, cx, cy, cs, ccounts, cp, edges, nonzero, 0, 0, 0, nullptr);
+  return features_batch("b2f_features_batch_grey", ctx, grey, 1, n_frames, ny, nx, hp, corner_cap, cx, cy, cs, ccounts, cp, edges, nonzero,
+                        0, 0, 0, nullptr);
 }
 
 }  // extern "C"

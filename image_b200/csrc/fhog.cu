@@ -697,33 +697,8 @@ int b2f_fhog_batch(b2f_ctx *ctx, const uint8_t *frames, int n_frames, int rows, 
   FhogGeom g;
   if (!fhog_geometry(rows, cols, cell_size, frp, fcp, g)) return B2F_OK;
   if (!hog) { set_error("b2f_fhog_batch: NULL output"); return B2F_EINVAL; }
-  B2F_CUDA(cudaSetDevice(ctx->device));
-  const size_t fin = (size_t)rows * cols * 3, fout = (size_t)g.out_nr * g.out_nc * 31;
-  const int C = frames_per_chunk(ctx, fin, n_frames), NCH = ceil_div(n_frames, C);
-  if ((rc = arena_reserve(ctx, fhog_scratch_bytes(C, g) + align256(fin * n_frames) + align256(fout * n_frames * 4))) != B2F_OK) return rc;
-  unsigned char *d_in = ctx->arena.get<unsigned char>(fin * n_frames);
-  float *d_out = ctx->arena.get<float>(fout * n_frames);
-  B2F_ARENA_CHECK(ctx);
-  const size_t mark = ctx->arena.off;
-  cudaStream_t st = ctx->stream;
-  if ((rc = pipe_prepare(ctx, 2 * NCH)) != B2F_OK) return rc;
-  for (int c = 0; c < NCH; c++) {          // upload c+1 | kernels c | download c-1 overlap
-    const int f0 = c * C, nf = std::min(C, n_frames - f0);
-    cudaEvent_t e_in = ctx->events[2 * c], e_done = ctx->events[2 * c + 1];
-    rc = B2F_OK;
-    if (cudaMemcpyAsync(d_in + fin * f0, frames + fin * f0, fin * nf, cudaMemcpyHostToDevice, ctx->s_in) != cudaSuccess ||
-        cudaEventRecord(e_in, ctx->s_in) != cudaSuccess || cudaStreamWaitEvent(st, e_in, 0) != cudaSuccess) rc = B2F_ECUDA;
-    ctx->arena.off = mark;
-    if (rc == B2F_OK) rc = fhog_device(ctx, d_in + fin * f0, nf, g, d_out + fout * f0, st);
-    if (rc == B2F_OK && (cudaEventRecord(e_done, st) != cudaSuccess || cudaStreamWaitEvent(ctx->s_out, e_done, 0) != cudaSuccess ||
-                         cudaMemcpyAsync(hog + fout * f0, d_out + fout * f0, fout * nf * 4, cudaMemcpyDeviceToHost, ctx->s_out) != cudaSuccess)) rc = B2F_ECUDA;
-    if (rc != B2F_OK) {
-      if (rc == B2F_ECUDA) set_error("b2f_fhog_batch: CUDA error in chunk %d: %s", c, cudaGetErrorString(cudaGetLastError()));
-      pipe_drain(ctx);
-      return rc;
-    }
-  }
-  return pipe_drain(ctx);
+  return features_batch("b2f_fhog_batch", ctx, frames, 3, n_frames, rows, cols, nullptr, 0, nullptr, nullptr, nullptr, nullptr,
+                        nullptr, nullptr, nullptr, cell_size, frp, fcp, hog);
 }
 
 int b2f_fhog_host(b2f_ctx *ctx, const uint8_t *rgb, int rows, int cols, int cell_size, int frp, int fcp, float *hog) {

@@ -18,6 +18,11 @@ int harris_corners_certified(b2f_ctx *ctx, const void *d_frames, bool u8, int n_
                              const b2f_harris_params *p, int cap, int *d_xy, float *d_strength, float *d_M9,
                              int *d_counts, float *d_R_out, cudaStream_t st);
 int harris_cert_stats(b2f_ctx *ctx, unsigned long long out[4], cudaStream_t st);
+// raster-ordered corner lists of frames resident on the device (output as b2f_harris_corners_dev): zero counts when no pixel
+// has a full window, else the certified path where p->exact and the fused kernel allow it, else response + NMS (d_R, when
+// NULL, from the arena)
+int harris_corners_device(b2f_ctx *ctx, const void *d_frames, bool u8, int n_frames, int nx, int ny, const b2f_harris_params *p,
+                          int cap, int *d_xy, float *d_strength, int *d_counts, float *d_R, cudaStream_t st);
 int harris_nms_device(b2f_ctx *ctx, const float *d_R, int n_frames, int nx, int ny, float Th, int radius, int cap,
                       int *d_xy, float *d_strength, int *d_counts, cudaStream_t st);
 // bit mask [n_frames][ny][wpr] -> exclusive per-row offsets of the set bits (row_off) and per-frame totals (d_counts)

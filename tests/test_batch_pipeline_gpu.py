@@ -27,7 +27,7 @@ def _frames(n, ny=150, nx=210):
 def test_canny_batch_chunked_equals_oracle(oracle, small_chunks):
     from image_b200.canny import canny_batch
     f = _frames(8)
-    edges, nz = canny_batch(f, ctx=small_chunks)                   # chunks of 3, 3, 2 frames
+    edges, nz = canny_batch(f, ctx=small_chunks)                   # chunks of 1, 3, 3, 1 frames
     one, nz1 = canny_batch(f)                                       # default context: a single chunk
     assert np.array_equal(edges, one) and np.array_equal(nz, nz1)
     for i in (0, 3, 7):
