@@ -196,6 +196,32 @@ int features_batch(const char *who, b2f_ctx *ctx, const uint8_t *rgb, int channe
   }
   if (do_c) for (int f = 0; f < n_frames; f++) nonzero[f] = p_nz[f];
   if (!do_h) return B2F_OK;
+  // A count of -1: the certified path had more candidates than corner_cap record slots (it sizes them by the caller's cap),
+  // so its list and count are unknown — although the frame may have no more than corner_cap corners — or a corner ties
+  // its left neighbour exactly, which only the reference's row scan settles.  Such frames run again through the staged
+  // kernels, whose NMS counts every corner; the grey plane of an RGB frame is derived once more from d_rgb, which still
+  // holds the whole batch.
+  for (int f = 0; f < n_frames; f++) {
+    if (p_cnt[f] >= 0) continue;
+    ctx->arena.region(mark_h, mark_c);
+    const unsigned char *g = d_rgb + fin * f;
+    if (channels == 3) {
+      const int al = ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(d_grey2[0])) & 15) == 0;
+      rgb_to_grey_kernel<<<(unsigned)((plane + 4095) / 4096), 256, 0, st>>>(g, d_grey2[0], plane, al);
+      B2F_LAUNCH_CHECK(ctx);
+      g = d_grey2[0];
+    }
+    b2f_harris_params q = *hp;
+    q.exact = 1;
+    const size_t o = (size_t)f * corner_cap;
+    if ((rc = harris_corners_device(ctx, g, true, 1, nx, ny, &q, corner_cap, d_xy + o, d_s + o, d_cnt + f, nullptr, st)) != B2F_OK) return rc;
+    if (SPEC > 0) {
+      B2F_CUDA(cudaMemcpyAsync(p_xy + (size_t)f * SPEC, d_xy + o, sizeof(int) * SPEC, cudaMemcpyDeviceToHost, st));
+      B2F_CUDA(cudaMemcpyAsync(p_s + (size_t)f * SPEC, d_s + o, sizeof(float) * SPEC, cudaMemcpyDeviceToHost, st));
+    }
+    B2F_CUDA(cudaMemcpyAsync(p_cnt + f, d_cnt + f, sizeof(int), cudaMemcpyDeviceToHost, st));
+    B2F_CUDA(cudaStreamSynchronize(st));
+  }
   bool over = false, deep = false;
   for (int f = 0; f < n_frames; f++) {
     int m = p_cnt[f];

@@ -172,6 +172,75 @@ nms_bitmask_kernel(const float *__restrict__ R, unsigned *__restrict__ mask, int
   }
 }
 
+// The row scan of harris.cpp:170-243 begins by walking down the leading run of the row (:175-176): it passes over every
+// pixel that is below the threshold, marked by the rows above, or not above its left neighbour.  A window maximum is passed
+// over only if its left neighbour ties it exactly, and then whether the walk gets there depends on the whole row prefix
+// and on the marks of the rows above.  The window predicate settles x == radius only.  One block per frame looks for any
+// other kept pixel tied with its left neighbour — exact ties at a maximum are rare: plateaus, or ridges of equal values
+// along straight edges when k < 0 — and, if there is one, one thread scans the frame again in the reference's order with
+// its skip mask and rewrites the frame's list and count.
+__global__ void __launch_bounds__(256)
+nms_tie_rescan_kernel(const float *__restrict__ R, const unsigned *__restrict__ mask, unsigned char *__restrict__ skip_all,
+                      int nx, int ny, int words_per_row, float Th, int radius, int cap, int *__restrict__ xy,
+                      float *__restrict__ strength, int *__restrict__ counts) {
+  __shared__ int tie;
+  const int f = blockIdx.x;
+  const size_t plane = (size_t)nx * ny;
+  const float *Rf = R + (size_t)f * plane;
+  const unsigned *mf = mask + (size_t)f * ny * words_per_row;
+  if (threadIdx.x == 0) tie = 0;
+  __syncthreads();
+  for (size_t w = threadIdx.x; w < (size_t)ny * words_per_row; w += blockDim.x) {
+    unsigned bits = mf[w];
+    const int y = (int)(w / words_per_row), x0 = (int)(w % words_per_row) * 32;
+    while (bits) {
+      const int x = x0 + __ffs(bits) - 1;
+      bits &= bits - 1;
+      if (x > radius && Rf[(size_t)y * nx + x - 1] == Rf[(size_t)y * nx + x]) tie = 1;
+    }
+  }
+  __syncthreads();
+  if (!tie) return;
+  unsigned char *skip = skip_all + (size_t)f * plane;
+  for (size_t i = threadIdx.x; i < plane; i += blockDim.x) skip[i] = Rf[i] < Th;
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  int count = 0;
+  for (int i = radius; i < ny - radius; i++) {
+    const float *row = Rf + (size_t)i * nx;
+    unsigned char *srow = skip + (size_t)i * nx;
+    int j = radius;
+    while (j < nx - radius && (srow[j] || row[j - 1] >= row[j])) j++;
+    while (j < nx - radius) {
+      while (j < nx - radius && (srow[j] || row[j + 1] >= row[j])) j++;
+      if (j >= nx - radius) break;
+      int p1 = j + 2;                                          // right of the peak: smaller values are marked
+      while (p1 <= j + radius && row[p1] < row[j]) { srow[p1] = 1; p1++; }
+      if (p1 > j + radius) {
+        int p2 = j - 1;                                        // left: ties allowed
+        while (p2 >= j - radius && row[p2] <= row[j]) p2--;
+        if (p2 < j - radius) {
+          bool found = false;
+          for (int k = i + radius; !found && k > i; k--)        // rows below, backwards: values not above are marked
+            for (int l = j + radius; !found && l >= j - radius; l--) {
+              if (Rf[(size_t)k * nx + l] > row[j]) found = true;
+              else skip[(size_t)k * nx + l] = 1;
+            }
+          for (int k = i - radius; !found && k < i; k++)        // rows above: ties end it
+            for (int l = j - radius; !found && l <= j + radius; l++)
+              if (Rf[(size_t)k * nx + l] >= row[j]) found = true;
+          if (!found) {
+            if (count < cap) { xy[(size_t)f * cap + count] = i * nx + j; strength[(size_t)f * cap + count] = row[j]; }
+            count++;
+          }
+        }
+      }
+      j = p1;
+    }
+  }
+  counts[f] = count;
+}
+
 // Fast variant for a compile-time radius: separable window maximum first (row pass, column pass in
 // shared memory), so that only pixels equal to their window maximum — a handful per tile — run the
 // exact asymmetric predicate.  Same result as nms_bitmask_kernel.
@@ -781,9 +850,14 @@ harris_exact_patch_kernel(const void *__restrict__ frames, const float *__restri
           }
         if (ok && m > 0 && x == radius && sO[m * W + m - 1] >= val) ok = false;   // harris.cpp:173
       }
+      // harris.cpp:175-176 passes over every pixel of the row, from x = radius on, as long as each one is below the
+      // threshold, marked, or not above its left neighbour.  A window maximum is passed over only if its left neighbour
+      // ties it exactly, and then whether the scan got there depends on the whole row prefix: such a frame is left to
+      // the staged kernels (keep = 2 -> count -1).
+      const bool tie_left = ok && !certain && m > 0 && x > radius && sO[m * W + m - 1] == val;
       const size_t o = (size_t)f * cap + ci;
       strength[o] = val;
-      keep[o] = ok ? 1 : 0;
+      keep[o] = tie_left ? 2 : (ok ? 1 : 0);
       if (M9 && m >= 1)
         for (int dy = -1; dy <= 1; dy++)
           for (int dx = -1; dx <= 1; dx++) M9[o * 9 + (dy + 1) * 3 + dx + 1] = sO[(m + dy) * W + m + dx];
@@ -804,15 +878,16 @@ compact_kept_kernel(const int *__restrict__ cand_xy, const unsigned char *__rest
                     const float *__restrict__ cand_M9, const int *__restrict__ cand_cnt, int cand_cap,
                     int *__restrict__ xy, float *__restrict__ strength, float *__restrict__ M9, int *__restrict__ counts, int cap) {
   __shared__ int warp_tot[32];
-  __shared__ int carry;
+  __shared__ int carry, undecidable;
   const int f = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int n = min(cand_cnt[f], cand_cap);
-  if (threadIdx.x == 0) carry = 0;
+  if (threadIdx.x == 0) { carry = 0; undecidable = 0; }
   __syncthreads();
   for (int base = 0; base < n; base += 1024) {
     const int i = base + threadIdx.x;
     const size_t ci = (size_t)f * cand_cap + i;
     const int kflag = (i < n && keep[ci]) ? 1 : 0;
+    if (i < n && keep[ci] == 2) undecidable = 1;
     int incl = kflag;
     for (int o = 1; o < 32; o <<= 1) { int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
     if (lane == 31) warp_tot[warp] = incl;
@@ -834,8 +909,9 @@ compact_kept_kernel(const int *__restrict__ cand_xy, const unsigned char *__rest
     if (threadIdx.x == 1023) carry = pos + kflag;
     __syncthreads();
   }
-  // more candidates than record slots: the list is incomplete, say so (callers fall back or report B2F_ECAP)
-  if (threadIdx.x == 0) counts[f] = cand_cnt[f] > cand_cap ? -1 : carry;
+  // more candidates than record slots (the list is incomplete), or a corner the row scan may pass over: say so (callers
+  // rerun the frame through the staged kernels)
+  if (threadIdx.x == 0) counts[f] = (cand_cnt[f] > cand_cap || undecidable) ? -1 : carry;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -931,6 +1007,7 @@ int harris_nms_device(b2f_ctx *ctx, const float *d_R, int n_frames, int nx, int 
   const int wpr = ceil_div(nx, 32);
   unsigned *mask = ctx->arena.get<unsigned>((size_t)n_frames * ny * wpr);
   int *row_off = ctx->arena.get<int>((size_t)n_frames * ny);
+  unsigned char *skip = ctx->arena.get<unsigned char>((size_t)n_frames * nx * ny);
   B2F_ARENA_CHECK(ctx);
   size_t smem = sizeof(float) * (size_t)(NMS_TW + 2 * radius) * (NMS_TH + 2 * radius);
   if (smem > 200 * 1024) { set_error("harris: NMS radius %d too large", radius); return B2F_EUNSUP; }
@@ -949,6 +1026,8 @@ int harris_nms_device(b2f_ctx *ctx, const float *d_R, int n_frames, int nx, int 
   row_scan_kernel<<<n_frames, 1024, 0, st>>>(row_off, d_counts, ny);
   B2F_LAUNCH_CHECK(ctx);
   emit_corners_kernel<<<dim3(ceil_div(ny, 8), n_frames), 256, 0, st>>>(mask, row_off, d_R, d_xy, d_strength, nx, ny, wpr, cap);
+  B2F_LAUNCH_CHECK(ctx);
+  nms_tie_rescan_kernel<<<n_frames, 256, 0, st>>>(d_R, mask, skip, nx, ny, wpr, Th, radius, cap, d_xy, d_strength, d_counts);
   B2F_LAUNCH_CHECK(ctx);
   return B2F_OK;
 }

@@ -118,6 +118,7 @@ size_t harris_scratch_bytes(int n_frames, int nx, int ny, const b2f_harris_param
   size_t plane = align256((size_t)nx * ny * sizeof(float)) * n_frames;
   size_t b = plane /*R*/ + 5 * plane /*exact path: I,T,A,B,C*/;
   b += align256((size_t)n_frames * ny * ceil_div(nx, 32) * 4) + align256((size_t)n_frames * ny * 4);   // mask, row offsets
+  b += align256((size_t)n_frames * nx * ny);                                                          // skip mask of a rescan
   b += 3 * align256((size_t)n_frames * cap * 4) + align256(n_frames * 4) + align256((size_t)n_frames * cap * 36);
   b += harris_certified_scratch_bytes(n_frames, nx, ny, cap, true);
   if (p->gaussian != 0) {   // SII line buffers
@@ -184,7 +185,8 @@ static int harris_one(b2f_ctx *ctx, const float *d_I, int nx, int ny, const b2f_
   if (nms_runs) {
     B2F_CUDA(cudaMemcpyAsync(&n, d_cnt, sizeof(int), cudaMemcpyDeviceToHost, st));
     B2F_CUDA(cudaStreamSynchronize(st));
-    if (n < 0) {                                                     // candidate records overflowed (ties over large flat areas): staged path
+    if (n < 0) {                                                     // candidate records overflowed (ties over large flat areas), or a corner
+                                                                     // ties its left neighbour (harris_exact_patch_kernel): staged path
       ctx->arena.off = mark;
       return harris_one(ctx, d_I, nx, ny, p, sigma_i, MODE_STAGED, out);
     }
@@ -334,7 +336,8 @@ int b2f_harris_nms_dev(b2f_ctx *ctx, const float *d_R, int n_frames, int nx, int
     B2F_CUDA(cudaMemsetAsync(d_counts, 0, sizeof(int) * n_frames, st));
     return B2F_OK;
   }
-  size_t need = align256((size_t)n_frames * ny * ceil_div(nx, 32) * 4) + align256((size_t)n_frames * ny * 4) + 4096;
+  size_t need = align256((size_t)n_frames * ny * ceil_div(nx, 32) * 4) + align256((size_t)n_frames * ny * 4) +
+                align256((size_t)n_frames * nx * ny) + 4096;
   int rc = arena_reserve(ctx, need);
   if (rc != B2F_OK) return rc;
   return harris_nms_device(ctx, d_R, n_frames, nx, ny, threshold, radius, cap, d_xy, d_strength, d_counts, st);

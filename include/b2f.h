@@ -90,8 +90,9 @@ int b2f_harris_response_dev(b2f_ctx *ctx, const void *d_frames, int is_u8, int n
                             const b2f_harris_params *p, float *d_R, void *stream);
 /* Frames resident in HBM -> reference-identical corner lists, all on the device and asynchronous on `stream`:
  * d_xy[f*cap + i] = y*nx + x (raster order, harris.cpp:250-252), d_strength the reference's R there,
- * d_counts[f] the number of corners (may exceed cap: only cap are stored; -1 = the internal candidate records
- * overflowed, rerun with a larger cap).  d_R (optional, n_frames*nx*ny floats) receives the fp32 response planes of the
+ * d_counts[f] the number of corners (may exceed cap: only cap are stored; -1 = the certified path could not settle the
+ * frame's list: its candidate records, sized by cap, overflowed, or a corner ties its left neighbour exactly, where the
+ * reference's row scan decides; rerun with a larger cap or with params.exact = 1).  d_R (optional, n_frames*nx*ny floats) receives the fp32 response planes of the
  * certified path, in which pixels whose reference response is certainly below the threshold may hold -FLT_MAX
  * (b2f_harris_response_dev / _eps_dev return the plain planes).
  * strategy / precision / Nscales of `p` are not applied here (b2f_harris_host does them per frame). */

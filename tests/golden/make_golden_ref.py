@@ -16,6 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path[:0] = [ROOT, os.path.dirname(HERE)]
 
 from oracle import pyoracle as po  # noqa: E402
+import harris_cases  # noqa: E402
 import test_oracle_contour_lsd as tcl  # noqa: E402
 import test_oracle_dlib as tdl  # noqa: E402
 import test_oracle_harris_canny as thc  # noqa: E402
@@ -24,7 +25,7 @@ import test_oracle_harris_canny as thc  # noqa: E402
 def main():
     assert all(po.have_ref(w) for w in ("harris", "canny", "dlib", "otsu", "contour", "lsd")), "build oracle/_ref first"
     d, blur = {}, {}
-    for key, img, kw in list(thc.harris_random_cases()) + list(thc.harris_tiny_cases()):
+    for key, img, kw in list(thc.harris_random_cases()) + list(thc.harris_tiny_cases()) + list(harris_cases.reference_cases()):
         d[key] = po.digest(*po.harris_detect(img, impl="ref", **kw))
     for key, img in thc.canny_cases():
         blur[key] = po.canny_blur_ref(img, 2.0).astype(np.float32)

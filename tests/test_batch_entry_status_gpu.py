@@ -62,14 +62,18 @@ def test_harris_batch_refusals():
     assert rc == 0 and cnt[0] > 0
 
 
-def test_harris_batch_reports_a_frame_over_cap():
+def test_harris_batch_reports_a_frame_over_cap(oracle):
+    """B2F_ECAP, and counts[f] is the frame's true count (not cap + 1), also on the certified path, whose candidate
+    records are sized by the cap."""
     from image_b200._lib import B2F_ECAP
     noise = np.random.default_rng(11).integers(0, 256, (NY, NX), dtype=np.uint8)
     flat = np.full((NY, NX), 90, np.uint8)
     cap = 16
-    rc, _, _, _, cnt = _harris(np.stack([noise, flat]), cap, threshold=1.0, sigma_i=1.0)
-    assert rc == B2F_ECAP
-    assert cnt[0] >= cap + 1 and cnt[1] == 0, cnt
+    n_true = len(oracle.harris_detect(noise, threshold=1.0, sigma_i=1.0)[0])
+    for mode in (0, 1):
+        rc, _, _, _, cnt = _harris(np.stack([noise, flat]), cap, threshold=1.0, sigma_i=1.0, exact=mode)
+        assert rc == B2F_ECAP
+        assert cnt[0] == n_true > cap + 1 and cnt[1] == 0, (mode, cnt, n_true)
 
 
 def test_harris_batch_exact_modes_give_the_same_lists():

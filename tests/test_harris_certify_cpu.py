@@ -52,6 +52,54 @@ def test_fp32_chain_stays_within_the_certified_bound(oracle, name, grad):
         assert np.median(eps[sig] / scale[sig]) < 2e-2
 
 
+def _grid():
+    """(sigma_d, sigma_i, k) beyond the defaults: every sigma_i of the fused kernel, every sigma_d, every k."""
+    import harris_cases as H
+    out = [(1.0, float(s), 0.06) for s in H.SIGMA_I if H.fused_supported(64, 64, 1.0, s)]
+    out += [(float(d), s, 0.06) for d in H.SIGMA_D[1:] for s in (1.0, 1.3, 2.5)]
+    out += [(1.15, s, k) for k in H.K for s in (1.2, 2.5)]
+    return out
+
+
+def _worst_ratio(oracle, img, sigma_d, sigma_i, k, grad):
+    """max |R_fp32 - R_oracle| / eps over the interior, eps per 8x8 block as the kernel evaluates it (M = max |pixel|)."""
+    Rf, tr = E.fused_response(img, k=k, sigma_d=sigma_d, sigma_i=sigma_i, grad=grad)
+    Ro, _ = oracle.harris_response(img, grad=grad, measure=0, k=k, sigma_d=sigma_d, sigma_i=sigma_i)
+    ny, nx = img.shape
+    by, bx = ny // 8, nx // 8
+    T = tr[: by * 8, : bx * 8].reshape(by, 8, bx, 8).max(axis=(1, 3))
+    M = maximum_filter(np.abs(img.astype(np.float32)), size=8 + 24 + 1)[4: by * 8: 8, 4: bx * 8: 8]
+    eps = np.kron(E.eps(T, M, k), np.ones((8, 8), np.float32))
+    diff = np.abs(Rf[: by * 8, : bx * 8].astype(np.float64) - Ro[: by * 8, : bx * 8].astype(np.float64))
+    return float((diff / eps)[16:-16, 16:-16].max())
+
+
+@pytest.mark.parametrize("sigma_d,sigma_i,k", _grid())
+def test_bound_holds_beyond_the_default_parameters(oracle, sigma_d, sigma_i, k):
+    """The bound is derived for any k (through |k|) and any normalised taps: checked on every adversarial frame, both
+    gradients, over the sigma / k grid the certified path accepts (sigma_i of both window radii families, k = 0, k < 0)."""
+    worst = 0.0
+    for name, img in _frames().items():
+        for grad in (0, 1):
+            worst = max(worst, _worst_ratio(oracle, img, sigma_d, sigma_i, k, grad))
+    assert worst < 1.0, worst
+
+
+@pytest.mark.parametrize("sigma_i,k", [(1.0, 0.06), (1.3, -0.05), (2.5, 0.06), (2.5, 0.15)])
+def test_bound_holds_on_float_input(oracle, sigma_i, k):
+    """Float frames (where M is the largest |pixel| of the tile): [0, 1] images, 16-bit ranges, negative values and
+    non-integer values."""
+    rng = np.random.default_rng(4)
+    worst = 0.0
+    for name in ("noise_full_range", "checker_8px", "shapes", "step_corner"):
+        x = _frames()[name].astype(np.float32)
+        for img in (x / np.float32(255), x * np.float32(257), x - np.float32(128),
+                    x + rng.uniform(-0.5, 0.5, x.shape).astype(np.float32)):
+            for grad in (0, 1):
+                worst = max(worst, _worst_ratio(oracle, img.astype(np.float32), 1.15, sigma_i, k, grad))
+    assert worst < 1.0, worst
+
+
 def test_bound_fails_when_shrunk(oracle):
     """The check above has teeth: the bound is a worst-case one (every rounding at its maximum, all with the same sign)
     and sits a few hundred times above the observed error; divided by 1000 it is violated somewhere."""

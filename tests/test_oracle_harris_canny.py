@@ -99,6 +99,18 @@ def test_harris_tiny_images_match_reference(oracle, ref_digests):
         assert oracle.digest(*oracle.harris_detect(img, impl="oracle", **kw)) == ref_digests[key], key
 
 
+def test_harris_oracle_equals_reference_beyond_default_parameters(oracle, ref_digests):
+    """The parameter sets the GPU tests compare against the oracle (tests/harris_cases.py): other sigma_i (both sides of
+    the tap half-width boundaries 4/3 and 7/3), sigma_d and k (zero and negative), sub-pixel modes, strategies, scales,
+    float input — the oracle's lists and strengths are the reference's bit for bit."""
+    import harris_cases
+    keys = []
+    for key, img, kw in harris_cases.reference_cases():
+        assert oracle.digest(*oracle.harris_detect(img, impl="oracle", **kw)) == ref_digests[key], key
+        keys.append(key)
+    assert len(keys) == len(set(keys)) > 60
+
+
 def test_canny_oracle_equals_reference_shim(oracle, golden, ref_digests):
     """The restatement (direct circular convolution) against the reference's own tools.c driven by
     the DFT shim: blurred planes may differ in float rounding for ~1e-7 of the pixels; edge maps
