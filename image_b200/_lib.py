@@ -112,6 +112,14 @@ def load():
         ("b2f_facedet_host_r32", [vp, vp, vp, C.c_size_t, C.c_int, C.c_int, C.c_int, ip, vp]),
         ("b2f_facedet_batch_rgb", [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp]),
         ("b2f_facedet_dev", [vp, vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, vp, vp]),
+        ("b2f_darknet_model_create", [vp, vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
+        ("b2f_darknet_model_free", [vp]),
+        ("b2f_darknet_model_dims", [vp, vp]),
+        ("b2f_darknet_detect_batch_rgb", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, vp, vp, vp]),
+        ("b2f_darknet_detect_dev", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_float, C.c_float, vp, vp, vp, vp]),
+        ("b2f_darknet_classify_batch_rgb", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
+        ("b2f_darknet_classify_dev", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
+        ("b2f_darknet_layer_dev", [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_size_t, vp, vp]),
     ]:
         if hasattr(lib, name):
             getattr(lib, name).argtypes = args
@@ -183,4 +191,6 @@ EXPORTS = [
     "b2f_contour_edge_points_host", "b2f_contour_edge_points_batch_u8", "b2f_contour_edge_points_dev",
     "b2f_nlmeans_resolve", "b2f_nlmeans_host_r32", "b2f_nlmeans_dev",
     "b2f_facedet_model_create", "b2f_facedet_model_free", "b2f_facedet_host_r32", "b2f_facedet_batch_rgb", "b2f_facedet_dev",
+    "b2f_darknet_model_create", "b2f_darknet_model_free", "b2f_darknet_model_dims", "b2f_darknet_detect_batch_rgb",
+    "b2f_darknet_detect_dev", "b2f_darknet_classify_batch_rgb", "b2f_darknet_classify_dev", "b2f_darknet_layer_dev",
 ]

@@ -306,6 +306,66 @@ int b2f_facedet_batch_rgb(b2f_ctx *ctx, const b2f_facedet_model *model, const ui
 int b2f_facedet_dev(b2f_ctx *ctx, const b2f_facedet_model *model, const uint8_t *d_frames, int n_frames, int width, int height,
                     int *n_faces, int32_t *faces, int32_t *layer_max, int32_t *cand, int cand_cap, int *n_cand, void *stream);
 
+/* ---------------------------------------------------------------------- darknet ----
+ * YOLO detection and ImageNet classification of image.darknet (darknet_test_detector and darknet_predict_classifier),
+ * bit-identical to the reference built with gcc -O2 on x86-64 (DESIGN.md §4.13, §5).  Convolutions sum in the reference's
+ * exact order on the CUDA cores.  The library ships no weights: the model is built from a cfg and .weights file that the
+ * caller parsed (image_b200/darknet.py, or the package's own parse_network_cfg + load_weights in the R glue).
+ * b2f_darknet_layer: one cfg section.  type is B2F_DN_*; B2F_DN_OTHER (0) is a section the engine does not run, named
+ *   by `name` in the error.  conv: filters, size, stride, pad (padding in pixels), batch_normalize, activation
+ *   (B2F_DN_LINEAR / B2F_DN_LEAKY), biases [filters], scales / rolling_mean / rolling_variance [filters] when
+ *   batch_normalize, weights [filters][c][size][size] with n_weights floats.  maxpool: size, stride, pad.  softmax:
+ *   groups (must be 1), temperature.  region: classes, coords (must be 4), num, softmax, anchors [2 num].  tree != 0
+ *   marks a softmax tree (unsupported).  avgpool and cost read no field.
+ * b2f_darknet_model_create: checks the whole network at net_w x net_h (3 channels), and returns B2F_EINVAL with a message
+ *   naming the layer for any unsupported layer or parameter (route, reorg, connected, dropout, crop, activations other
+ *   than leaky / linear, softmax trees, a weights array shorter or longer than the layer needs).  Conv, maxpool and
+ *   avgpool layers run on the GPU; softmax, region and cost may only follow them.  The weights go to ctx's device once.
+ * b2f_darknet_model_dims: dims[0] = boxes per frame of the region layer (l.w * l.h * l.n, 0 without one), dims[1] = its
+ *   classes, dims[2] = net.outputs (the length of the network output at net_w x net_h).
+ * b2f_darknet_detect_*: frames [n][height][width][3] u8 -> per frame, after resize_image to net_w x net_h, the forward pass,
+ *   get_region_boxes and do_nms_sort at nms .4: probs [n][boxes][classes + 1], boxes [n][boxes][4] (x, y, w, h) and
+ *   count [n] = the boxes whose best class is above thresh.  hier_thresh only matters for softmax trees (not supported).
+ * b2f_darknet_classify_*: resize_min(frame, net_w), the forward pass at that size (resize != 0) or at net_w x net_h on the
+ *   first 3 net_w net_h floats of the resized planes (resize == 0), and top_k: index [n][top], prob [n][top].  top must be
+ *   in 1..net.outputs.  The network may have no region layer.  With resize == 0, a frame whose resized planes hold fewer
+ *   than net_w net_h pixels (a cfg taller than wide) gives B2F_EUNSUP: the reference reads past its buffer there.
+ * The _batch_rgb forms take host frames (chunked, the upload of the next chunk overlapping the current one); the _dev forms
+ *   frames in HBM, on `stream` (NULL = ctx stream), and return when the host outputs are written.
+ * b2f_darknet_layer_dev: the output of layer `layer` (-1 = the network input: the resized planes) for mode 0 = detect,
+ *   1 = classify with resize, 2 = classify without; out [n][c][h][w] floats with dims = (c, h, w).  out = NULL returns only
+ *   dims; out_len must hold n c h w floats.  Region and softmax layers give the reference's l.output; cost layers are
+ *   refused. */
+enum { B2F_DN_OTHER = 0, B2F_DN_CONV = 1, B2F_DN_MAXPOOL = 2, B2F_DN_AVGPOOL = 3, B2F_DN_SOFTMAX = 4, B2F_DN_REGION = 5,
+       B2F_DN_COST = 6 };
+enum { B2F_DN_LINEAR = 0, B2F_DN_LEAKY = 1, B2F_DN_ACT_OTHER = 2 };
+typedef struct b2f_darknet_layer {
+  int type;
+  const char *name;
+  int filters, size, stride, pad, batch_normalize, activation;
+  int groups;
+  float temperature;
+  int classes, coords, num, softmax, tree;
+  const float *biases, *scales, *rolling_mean, *rolling_variance, *weights;
+  size_t n_weights;
+  const float *anchors;
+} b2f_darknet_layer;
+typedef struct b2f_darknet_model b2f_darknet_model;
+int b2f_darknet_model_create(b2f_ctx *ctx, const b2f_darknet_layer *layers, int n_layers, int net_w, int net_h,
+                             b2f_darknet_model **model);
+void b2f_darknet_model_free(b2f_darknet_model *model);
+int b2f_darknet_model_dims(const b2f_darknet_model *model, int *dims);
+int b2f_darknet_detect_batch_rgb(b2f_ctx *ctx, const b2f_darknet_model *model, const uint8_t *frames, int n_frames, int width,
+                                 int height, float thresh, float hier_thresh, float *probs, float *boxes, int *count);
+int b2f_darknet_detect_dev(b2f_ctx *ctx, const b2f_darknet_model *model, const uint8_t *d_frames, int n_frames, int width,
+                           int height, float thresh, float hier_thresh, float *probs, float *boxes, int *count, void *stream);
+int b2f_darknet_classify_batch_rgb(b2f_ctx *ctx, const b2f_darknet_model *model, const uint8_t *frames, int n_frames, int width,
+                                   int height, int resize, int top, int *index, double *prob);
+int b2f_darknet_classify_dev(b2f_ctx *ctx, const b2f_darknet_model *model, const uint8_t *d_frames, int n_frames, int width,
+                             int height, int resize, int top, int *index, double *prob, void *stream);
+int b2f_darknet_layer_dev(b2f_ctx *ctx, const b2f_darknet_model *model, const uint8_t *d_frames, int n_frames, int width,
+                          int height, int mode, int layer, float *out, size_t out_len, int *dims, void *stream);
+
 #ifdef __cplusplus
 }
 #endif
